@@ -4,11 +4,12 @@
 Tolerance (stated, SURVEY.md §8d / reference test_dual.py:35-36): the WHOLE split sequence exact unless the oracle's
 own best-vs-runner-up margin at the first differing split is below 1e-5 relative (helpers.compare_trees); gains /
 sums / leaf values within rel 1e-5.  The histogram kernel sums 30-bit fixed-point gradients exactly (int32 hi/lo
-shared-memory atomics -> int64 pool), so the only error left is the one rounding per row: max|g| * 2^-31."""
+shared-memory atomics -> int64 pool): histograms must EQUAL helpers.fixed_point_hist, and differ from the oracle's fp64
+sums by at most the one rounding per row, 2^-(k+1) per row of the cell."""
 import numpy as np
 import pytest
 
-from helpers import compare_trees, synth_identity
+from helpers import assert_hist_equal, cell_counts, compare_trees, fixed_point_hist, synth_identity
 
 pytestmark = pytest.mark.gpu
 
@@ -38,13 +39,14 @@ def test_histogram_matches_oracle(mods, n, f, nidx):
     L = _learner(lgb, lay, num_leaves=4)
     idx = None if nidx is None else np.sort(np.random.default_rng(7).choice(n, nidx, replace=False)).astype(np.int32)
     got, ms = L.construct_histogram(g, h, idx)
+    # every cell IS the exact sum of the rows' fixed-point values (integer arithmetic end to end)
+    _, exact, (kg, kh) = fixed_point_hist(bins, idx, g, h)
+    assert_hist_equal(got, exact, "general-hessian kernel")
+    # and the fixed point rounds each row once: within count * 2^-(k+1) of the oracle's fp64 sums
     want = orc.construct_histogram(lay, idx, g, h)
-    # empty bins are exactly zero; populated bins agree to fp32-partial accuracy
-    assert np.array_equal(got == 0, want == 0) or np.allclose(got, want, rtol=1e-5, atol=1e-4)
-    scale = np.maximum(np.abs(want), 1.0)
-    assert np.max(np.abs(got - want) / scale) < 2e-5
-    # hessian column sums equal the exact total within fp32 accumulation error
-    np.testing.assert_allclose(got[:, :, 1].sum(axis=1), want[:, :, 1].sum(axis=1), rtol=1e-5)
+    cnt = cell_counts(bins, idx)
+    assert (np.abs(got[..., 0] - want[..., 0]) <= cnt * 2.0 ** -(kg + 1)).all()
+    assert (np.abs(got[..., 1] - want[..., 1]) <= cnt * 2.0 ** -(kh + 1)).all()
 
 
 @pytest.mark.parametrize("n,f,nidx", [(20000, 40, None), (50000, 70, 12345), (100, 64, 33), (70000, 33, None), (257, 1, None)])
@@ -58,11 +60,12 @@ def test_constant_hessian_histogram_matches_oracle(mods, n, f, nidx):
     L = _learner(lgb, lay, const_hess=True, num_leaves=4)
     idx = None if nidx is None else np.sort(np.random.default_rng(7).choice(n, nidx, replace=False)).astype(np.int32)
     got, ms = L.construct_histogram(g, h, idx)
+    _, exact, (kg, kh) = fixed_point_hist(bins, idx, g, h, const_hess=True)
+    assert_hist_equal(got, exact, "constant-hessian kernel")     # hessian cells: count * llrint(h0 * 2^kh) exactly
     want = orc.construct_histogram(lay, idx, g, h)
-    assert np.array_equal(got == 0, want == 0)
-    np.testing.assert_allclose(got[:, :, 1], want[:, :, 1], rtol=1e-7)          # counts * h0 (h0 quantized to 30 bits)
-    scale = np.maximum(np.abs(want[:, :, 0]), 1.0)
-    assert np.max(np.abs(got[:, :, 0] - want[:, :, 0]) / scale) < 1e-6
+    cnt = cell_counts(bins, idx)
+    assert (np.abs(got[..., 0] - want[..., 0]) <= cnt * 2.0 ** -(kg + 1)).all()
+    assert (np.abs(got[..., 1] - want[..., 1]) <= cnt * 2.0 ** -(kh + 1)).all()
 
 
 def test_histogram_is_deterministic(mods):
