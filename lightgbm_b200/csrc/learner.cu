@@ -1285,6 +1285,12 @@ class Predictor {
       for (int i = 0; i < L - 1; ++i, ++ni) {
         PNodeA a; PNodeB b;
         a.threshold = threshold[ni]; a.feature = split_feature[ni]; b.left = left_child[ni]; b.right = right_child[ni];
+        // LGBM_BoosterPredictForMat reads rows through RowPairFunctionFromDenseMatrix, which drops every |x| <= kZeroThreshold
+        // (c_api.cpp:2864): the tree sees 0.0 for such a value.  A threshold inside [-kZ, kZ) moved just outside the band
+        // makes the plain `x <= t` of the walk equal `(|x| <= kZ ? 0.0 : x) <= t` for every x, so the kernels compare the
+        // raw value and need no instruction for the band.  Bin bounds put -kZ here (bin.cpp:191,195,279).
+        if (a.threshold >= -kZeroBound && a.threshold < 0.0) a.threshold = std::nextafter(-kZeroBound, -INFINITY);
+        else if (a.threshold >= 0.0 && a.threshold < kZeroBound) a.threshold = kZeroBound;
         a.decision = static_cast<int32_t>(decision_type[ni]) & 0xff;
         REQUIRE(!(a.decision & 1), "categorical splits are not supported");
         REQUIRE(a.feature >= 0 && a.feature <= max_feature_idx, "split feature out of range");

@@ -223,16 +223,30 @@ class Model:
             self._pred = h
         return self._pred
 
-    def predict_raw(self, X: np.ndarray, return_ms: bool = False):
-        X = np.ascontiguousarray(X)
-        if X.dtype not in (np.float32, np.float64):
-            X = X.astype(np.float64)
-        assert X.ndim == 2
-        out = np.empty(X.shape[0], np.float64)
+    def predict_raw(self, X, return_ms: bool = False, data_shape: tuple | None = None, out=None):
+        """Raw scores of the rows of X.  `X`: a host row-major matrix, or a (DeviceArray, dtype) pair already in HBM (then
+        pass data_shape = (rows, cols)).  `out`: None for a host float64 array, or a DeviceArray of at least 8 * rows bytes
+        that receives the scores and is returned.  Input and output both on the device run as one launch, nothing staged."""
+        if isinstance(X, tuple):
+            dev, dtype = X
+            rows, cols = (int(v) for v in data_shape)
+            src, code, on_dev = dev.ptr, (0 if np.dtype(dtype) == np.float32 else 1), 1
+        else:
+            X = np.ascontiguousarray(X)
+            if X.dtype not in (np.float32, np.float64):
+                X = X.astype(np.float64)
+            assert X.ndim == 2
+            (rows, cols), src, code, on_dev = X.shape, _p(X), (0 if X.dtype == np.float32 else 1), 0
+        if out is None:
+            res = np.empty(rows, np.float64)
+            dst, out_dev = _p(res), 0
+        else:
+            assert out.nbytes >= 8 * rows
+            res, dst, out_dev = out, out.ptr, 1
         ms = C.c_float(0)
-        check(lib().LGBMB200_PredictorPredict(self._predictor(), _p(X), C.c_int32(0 if X.dtype == np.float32 else 1), C.c_int32(X.shape[0]),
-                                              C.c_int32(X.shape[1]), C.c_int32(0), _p(out), C.c_int32(0), C.byref(ms)))
-        return (out, float(ms.value)) if return_ms else out
+        check(lib().LGBMB200_PredictorPredict(self._predictor(), src, C.c_int32(code), C.c_int32(rows), C.c_int32(cols),
+                                              C.c_int32(on_dev), dst, C.c_int32(out_dev), C.byref(ms)))
+        return (res, float(ms.value)) if return_ms else res
 
     def predict(self, X: np.ndarray, raw_score: bool = False) -> np.ndarray:
         raw = self.predict_raw(X)

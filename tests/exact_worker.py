@@ -1,5 +1,6 @@
-"""Seeded cases of the bit-exact histogram tests, and a subprocess entry point for the ones that need a developer
-switch read once per process (LGBMB200_SPLIT_K, LGBMB200_DEBUG: lightgbm_b200/csrc/learner.cu).
+"""Seeded cases of the bit-exact histogram and prediction tests, and a subprocess entry point for the ones that run under
+a developer switch (LGBMB200_SPLIT_K, LGBMB200_DEBUG, LGBMB200_PRED_PASS: lightgbm_b200/csrc/learner.cu), so that the
+setting cannot reach other tests.
 
     python tests/exact_worker.py <case name> <out.npz>
 
@@ -80,9 +81,24 @@ def train_case(lgb, name):
     return L, lay, t, part, hists
 
 
+def predict_case(dtype, seed=31, ncol=40):
+    """A 33-tree synthetic model and rows on and next to its thresholds (tests/helpers.py)."""
+    import helpers as H
+    rng = np.random.default_rng(seed)
+    m = H.synthetic_model(rng, 33, ncol, features=[0, ncol - 1] + list(rng.integers(0, ncol, 8)))
+    return m, H.boundary_matrix(H.model_columns(m, ncol, dtype == np.float64), 300, rng, dtype)
+
+
 def main():
     name, out = sys.argv[1], sys.argv[2]
     import lightgbm_b200 as lgb
+    if name == "predict":
+        res = {}
+        for dt in (np.float32, np.float64):
+            m, X = predict_case(dt)
+            res[np.dtype(dt).name] = m.predict_raw(X)
+        np.savez(out, **res)
+        return
     if name.startswith("occupancy_"):
         _, sign, kernel = name.split("_")
         bins, g, h = occupancy_data(sign)

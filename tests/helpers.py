@@ -208,3 +208,260 @@ def exact_grad(values, bits=10, bound_log2=6):
 def exact_hess(rng, n):
     """Multiples of 2^-6 in [2^-3, 4]."""
     return (rng.integers(8, 257, n) * 2.0 ** -6).astype(np.float32)
+
+
+# ---- plain restatements of the rows either side of the path (DESIGN.md §4.8, §4.9) ---------------------------------
+# The value -> bin pass and the predictor claim bit identity with LGBM_DatasetCreateFromMat and LGBM_BoosterPredictForMat.
+# These restate both in float64 numpy, and the generators below build inputs that sit on and next to every bin bound and
+# every threshold, where a `<` for a `<=` or a missing float rounding step would show.
+
+K_ZERO = float(np.float32(1e-35))            # kZeroThreshold (meta.h:56): the float literal, widened
+MISSING_NONE, MISSING_ZERO, MISSING_NAN = 0, 1, 2
+FLT_MAX = float(np.finfo(np.float32).max)
+
+
+def value_to_bin_reference(X, meta, upper_bounds):
+    """The uint8 [rows, num_columns] matrix LGBM_DatasetCreateFromMat stores for the float matrix X under a fitted layout
+    (`Binner.layout_meta()` keys) and its bin upper bounds.  A feature's bin is BinMapper::ValueToBin (bin.h:612-637):
+    the count of searchable bounds below (double)x, with num_bin - 1 searchable bounds, one fewer when the last bin is the
+    NaN bin; NaN goes to that bin, or is read as 0.0 under the other missing types.  FeatureGroup::PushData stores nothing
+    at the most frequent bin and lo + bin - (mfb == 0) elsewhere; a later sub-feature of a bundle overwrites an earlier one."""
+    X = np.asarray(X)
+    out = np.zeros((X.shape[0], int(meta["num_columns"])), np.uint8)
+    for f in range(int(meta["num_features"])):
+        nb, mt, mfb = int(meta["feat_num_bin"][f]), int(meta["feat_missing_type"][f]), int(meta["feat_most_freq_bin"][f])
+        x = X[:, int(meta["feat_real_index"][f])].astype(np.float64)
+        nan = np.isnan(x)
+        searchable = nb - 1 - (1 if mt == MISSING_NAN else 0)
+        b = np.searchsorted(np.asarray(upper_bounds[f], np.float64)[:searchable], np.where(nan, 0.0, x), side="left")
+        if mt == MISSING_NAN:
+            b[nan] = nb - 1
+        keep = b != mfb
+        out[keep, int(meta["feat_column"][f])] = (int(meta["feat_lo"][f]) + b[keep] - (1 if mfb == 0 else 0)).astype(np.uint8)
+    return out
+
+
+def predict_raw_reference(model, X):
+    """LGBM_BoosterPredictForMat raw scores of a numerical model (lightgbm_b200.Model) for the float matrix X.  The rows are
+    read through RowPairFunctionFromDenseMatrix, which drops every value with |x| <= kZeroThreshold (c_api.cpp:2864), so
+    the trees see 0.0 there; each node decides as NumericalDecision does (tree.h:337-355); the leaf values are added in
+    float64, one tree at a time in model order, starting from 0 (GBDT::PredictRaw)."""
+    X = np.asarray(X).astype(np.float64)
+    X = np.where(np.abs(X) <= K_ZERO, 0.0, X)                 # NaN compares false and stays
+    n = X.shape[0]
+    out = np.zeros(n, np.float64)
+    for t in model.trees:
+        if t.num_leaves <= 1:
+            out += t.leaf_value[0]
+            continue
+        node = np.zeros(n, np.int64)
+        live = np.arange(n)
+        while live.size:
+            nd = node[live]
+            v = X[live, t.split_feature[nd]]
+            dt = t.decision_type[nd].astype(np.int64)
+            mt = (dt >> 2) & 3
+            nan = np.isnan(v)
+            v = np.where(nan & (mt != MISSING_NAN), 0.0, v)
+            to_default = ((mt == MISSING_ZERO) & (v >= -K_ZERO) & (v <= K_ZERO)) | ((mt == MISSING_NAN) & nan)
+            left = np.where(to_default, (dt & 2) != 0, v <= t.threshold[nd])
+            node[live] = np.where(left, t.left_child[nd], t.right_child[nd])
+            live = live[node[live] >= 0]
+        out += t.leaf_value[~node]
+    return out
+
+
+# ---- adversarial inputs: values on and next to bounds and thresholds ------------------------------------------------
+
+def f32_floor(t: float) -> float:
+    """The largest float32 <= the double t (what the device compares a float against)."""
+    with np.errstate(over="ignore"):
+        f = np.float32(t)
+    if float(f) > t:
+        f = np.nextafter(f, np.float32(-np.inf))
+    return float(f)
+
+
+def _f32_next(v: float, toward: float) -> float:
+    with np.errstate(over="ignore"):
+        return float(np.nextafter(np.float32(v), np.float32(toward)))
+
+
+def edge_values(float64: bool) -> list:
+    """Values that probe the zero band, the denormals and the ends of the range whatever the bounds are."""
+    v = [0.0, -0.0, np.nan, np.inf, -np.inf, FLT_MAX, -FLT_MAX]
+    for s in (1.0, -1.0):
+        v += [s * K_ZERO, s * _f32_next(K_ZERO, np.inf), s * _f32_next(K_ZERO, 0.0),
+              s * float(np.nextafter(K_ZERO, np.inf)), s * float(np.nextafter(K_ZERO, 0.0)), s * 5e-36,
+              s * float(np.float32(2.0 ** -149)), s * float(np.float32(1e-40)), s * float(np.float32(1e-38))]
+        if float64:
+            v += [s * 1e-320, s * 1e-310, s * 1e300]
+    return v
+
+
+def boundary_values(bounds, float64: bool) -> np.ndarray:
+    """Per-feature adversarial values for the finite bounds (or thresholds) `bounds`: each bound t, its float64
+    neighbours, the largest float <= t and the float above that, values below the first and above the last, and
+    edge_values().  Distinct by bit pattern, so +0.0 and -0.0 both stay."""
+    b = np.asarray([x for x in np.asarray(bounds, np.float64) if np.isfinite(x)])
+    v = list(edge_values(float64))
+    for t in b:
+        lo = f32_floor(t)
+        v += [t, float(np.nextafter(t, np.inf)), float(np.nextafter(t, -np.inf)), lo, _f32_next(lo, np.inf)]
+    if len(b):
+        v += [b.min() - 1.0 - abs(b.min()), b.max() + 1.0 + abs(b.max())]
+    a = np.asarray(v, np.float64)
+    return a[np.unique(a.view(np.int64), return_index=True)[1]]
+
+
+def boundary_matrix(columns, rows, rng, dtype) -> np.ndarray:
+    """[max(rows, longest column), len(columns)] matrix of `dtype`: column j lists every value of columns[j] once (in a
+    random order), then random repeats of them."""
+    n = max([rows] + [len(c) for c in columns])
+    X = np.empty((n, len(columns)), np.float64)
+    for j, c in enumerate(columns):
+        c = np.asarray(c, np.float64)
+        X[:, j] = np.concatenate([rng.permutation(c), rng.choice(c, n - len(c))])
+    with np.errstate(over="ignore", under="ignore"):
+        return np.ascontiguousarray(X.astype(dtype))
+
+
+def threshold_pool(rng, k=16) -> np.ndarray:
+    """Split thresholds: exact floats, doubles no float equals (midpoints of adjacent floats), the zero band (+-kZ, 0,
+    values inside it, the double below -kZ), +-1e300 and +-FLT_MAX."""
+    f = (rng.normal(size=k) * 10.0 ** rng.integers(-3, 4, k)).astype(np.float32)
+    mids = (f.astype(np.float64) + np.nextafter(f, np.float32(np.inf)).astype(np.float64)) / 2.0
+    band = [K_ZERO, -K_ZERO, 0.0, -0.0, 5e-36, -5e-36, float(np.nextafter(-K_ZERO, -np.inf)), float(np.nextafter(K_ZERO, 0.0)),
+            float(np.nextafter(-K_ZERO, 0.0))]
+    return np.concatenate([f.astype(np.float64), mids, band, [1e300, -1e300, FLT_MAX, -FLT_MAX]])
+
+
+def _tree_links(pick_leaf, L):
+    """Child arrays of a tree grown as Tree::Split grows one (tree.h:543-585): split `node` turns leaf pick_leaf(node)
+    into an internal node whose left child keeps that leaf id and whose right child is the new leaf node + 1."""
+    n = L - 1
+    lc, rc = np.zeros(n, np.int32), np.zeros(n, np.int32)
+    parent = np.full(L, -1, np.int64)
+    for node in range(n):
+        leaf = pick_leaf(node)
+        p = parent[leaf]
+        if p >= 0:
+            if lc[p] == ~leaf:
+                lc[p] = node
+            else:
+                rc[p] = node
+        lc[node], rc[node] = ~leaf, ~(node + 1)
+        parent[leaf] = parent[node + 1] = node
+    return lc, rc
+
+
+def synthetic_tree(rng, shape, features, pool, decision_types=None):
+    """A ModelTree of `shape`: "random" (2..64 leaves), "chain" (255 leaves, 254 deep, zig-zag), "balanced" (2..128
+    leaves, full levels) or "leaf" (a single leaf).  Split features from `features`, thresholds from `pool`, decision
+    types from `decision_types` (default: all six numerical ones).  Leaf values span 16 decades, so the order in which
+    they are added changes the sum."""
+    from lightgbm_b200.model import ModelTree
+    if shape == "leaf":
+        L, lc, rc = 1, np.zeros(0, np.int32), np.zeros(0, np.int32)
+    elif shape == "random":
+        L = int(rng.integers(2, 65))
+        lc, rc = _tree_links(lambda node: int(rng.integers(0, node + 1)), L)
+    elif shape == "balanced":
+        depth = int(rng.integers(1, 8))
+        L = 1 << depth
+        order = [j for d in range(depth) for j in range(1 << d)]
+        lc, rc = _tree_links(lambda node: order[node], L)
+    else:
+        L = 255
+        last = [0]
+
+        def pick(node):                          # one of the two children of the previous split
+            if node > 0 and rng.random() < 0.5:
+                last[0] = node
+            return last[0]
+        lc, rc = _tree_links(pick, L)
+    n = L - 1
+    dts = np.asarray(decision_types if decision_types is not None else [m << 2 | d for m in range(3) for d in (0, 2)], np.int8)
+    return ModelTree(L, rng.choice(np.asarray(features, np.int32), n).astype(np.int32), np.ones(n, np.float32),
+                     rng.choice(np.asarray(pool, np.float64), n), rng.choice(dts, n).astype(np.int8), lc, rc,
+                     rng.normal(size=L) * 10.0 ** rng.integers(-8, 8, L), np.ones(L), np.ones(L, np.int32),
+                     np.zeros(n), np.zeros(n), np.zeros(n, np.int32))
+
+
+def text_model(trees, ncol):
+    """Write the trees as model text and read it back (Model.to_string / Model.from_string), as a user's model arrives."""
+    from lightgbm_b200.model import Model
+    return Model.from_string(Model(trees=list(trees), max_feature_idx=ncol - 1).to_string())
+
+
+def synthetic_model(rng, num_trees, ncol, features=None, pool=None, shapes=("random", "chain", "balanced", "leaf")):
+    features = list(range(ncol)) if features is None else features
+    pool = threshold_pool(rng) if pool is None else pool
+    return text_model([synthetic_tree(rng, shapes[i % len(shapes)], features, pool) for i in range(num_trees)], ncol)
+
+
+def stump_grid_model(pool, ncol):
+    """One single-split tree per (threshold, decision type) pair, round-robin over the columns: with every column holding
+    every adversarial value, each value meets each threshold under each missing type and default direction."""
+    from lightgbm_b200.model import ModelTree
+    trees = []
+    dts = [m << 2 | d for m in range(3) for d in (0, 2)]
+    for i, (t, dt) in enumerate((t, dt) for t in pool for dt in dts):
+        trees.append(ModelTree(2, np.array([i % ncol], np.int32), np.ones(1, np.float32), np.array([t]), np.array([dt], np.int8),
+                               np.array([-1], np.int32), np.array([-2], np.int32), np.array([2.0 ** -(i % 40), -(3.0 ** (i % 23))]),
+                               np.ones(2), np.ones(2, np.int32), np.zeros(1), np.zeros(1), np.zeros(1, np.int32)))
+    return text_model(trees, ncol)
+
+
+def model_columns(model, ncol, float64):
+    """boundary_values() of every column from the thresholds the model splits it on."""
+    th = [[] for _ in range(ncol)]
+    for t in model.trees:
+        for f, v in zip(t.split_feature[:t.num_leaves - 1], t.threshold[:t.num_leaves - 1]):
+            th[int(f)].append(float(v))
+    return [boundary_values(c, float64) for c in th]
+
+
+# Binner features whose searchable bound counts hit every depth edge of search_bounds_smem (binning.cuh)
+BOUND_COUNTS = (0, 1, 2, 3, 4, 7, 8, 15, 16, 31, 32, 63, 64, 127, 128, 254)
+
+
+def binner_fit_matrix(rng, n=2000, dtype=np.float32):
+    """A float matrix to fit with min_data_in_bin=1 and feature_pre_filter=false.  k distinct positive values give k
+    searchable bounds (kZeroThreshold, then the k - 1 midpoints); a zero + NaN column gives a NaN-bin feature with none
+    searchable, a constant + NaN column one; mixed-sign columns put -kZ and kZ among the bounds; a continuous column
+    takes the equal-count branch of the bin finder."""
+    cols = []
+
+    def spread(vals):
+        vals = np.asarray(vals, np.float64)
+        return rng.permutation(np.concatenate([vals, rng.choice(vals, n - len(vals))]))
+    for r in BOUND_COUNTS[1:]:
+        cols.append(spread(np.unique(rng.uniform(0.5, 1000.0, 4 * r).astype(np.float32))[:r]))
+    cols.append(np.where(rng.random(n) < 0.5, 0.0, np.nan))                         # zero + NaN: no searchable bound
+    cols.append(np.where(rng.random(n) < 0.3, np.nan, 3.25))                        # constant + NaN: one
+    cols.append(spread(np.arange(-3.0, 4.0)))                                       # -3 .. 3: -kZ and kZ are bounds
+    cols.append(spread(np.concatenate([-np.unique(rng.uniform(1e-3, 50, 40).astype(np.float32)), [0.0]])))
+    c = rng.normal(size=n); c[rng.random(n) < 0.1] = np.nan; cols.append(c)          # continuous with NaN
+    c = rng.normal(size=n) * 1e-30; c[rng.random(n) < 0.3] = 0.0; cols.append(c)     # values near the zero band
+    return np.ascontiguousarray(np.stack(cols, axis=1).astype(dtype))
+
+
+def binner_sparse_matrix(rng, n=3000, c=24, dtype=np.float32):
+    """Mostly exclusive sparse columns (each row has one non-zero column), which feature bundling packs into shared
+    stored columns, next to two dense ones."""
+    X = np.zeros((n, c), np.float64)
+    owner = rng.permutation(np.concatenate([np.arange(c - 2), rng.integers(0, c - 2, n - (c - 2))]))     # every column used
+    X[np.arange(n), owner] = rng.choice(np.array([-2.5, -1.0, 0.5, 1.0, 2.0, 7.0]), n) * (1 + owner % 3)
+    X[:, c - 2] = rng.normal(size=n)
+    X[:, c - 1] = np.round(rng.normal(size=n) * 3)
+    return np.ascontiguousarray(X.astype(dtype))
+
+
+def binner_columns(meta, ub, ncol, float64):
+    """boundary_values() of every real column from its fitted searchable bounds (edge values alone for unused columns)."""
+    cols = [boundary_values([], float64) for _ in range(ncol)]
+    for f in range(int(meta["num_features"])):
+        nb, mt = int(meta["feat_num_bin"][f]), int(meta["feat_missing_type"][f])
+        cols[int(meta["feat_real_index"][f])] = boundary_values(ub[f][:nb - 1 - (1 if mt == MISSING_NAN else 0)], float64)
+    return cols
