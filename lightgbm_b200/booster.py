@@ -10,6 +10,7 @@ Two modes, matching the reference's `boosting_on_gpu_` switch (gbdt.cpp:110-135)
 """
 from __future__ import annotations
 
+import math
 import os
 import time
 from concurrent.futures import ThreadPoolExecutor
@@ -20,6 +21,7 @@ from .tree_learner import B200TreeLearner, Config, DeviceArray, Layout, Tree
 
 
 _POOL: ThreadPoolExecutor | None = None
+K_EPSILON = float(np.float32(1e-15))     # kEpsilon (meta.h:54): the float literal, widened
 
 
 def _host_threads() -> int:
@@ -69,15 +71,12 @@ class B200Booster:
         self.host_ms = {"gradients": 0.0, "train": 0.0, "score": 0.0}   # wall-clock split of update(), host mode
         assert objective in ("regression", "binary")
         self.objective, self.sigmoid = objective, float(sigmoid)
-        # BoostFromAverage (gbdt.cpp:328-350): RegressionL2loss::BoostFromScore = mean label;
-        # BinaryLogloss::BoostFromScore = log(p/(1-p))/sigmoid (binary_objective.hpp:139-165)
-        if not boost_from_average:
-            self.init_score = 0.0
-        elif objective == "regression":
-            self.init_score = float(np.mean(self.label, dtype=np.float64))
-        else:
-            pavg = min(max(float(np.mean(self.label > 0, dtype=np.float64)), 1e-15), 1 - 1e-15)
-            self.init_score = float(np.log(pavg / (1 - pavg)) / self.sigmoid)
+        # BoostFromAverage (gbdt.cpp:327-350): the scores start from the objective's init score, and tree 0 carries it as
+        # a bias, only when it is larger than kEpsilon
+        self.boost_from_average = bool(boost_from_average)
+        init = self._automatic_init_score() if boost_from_average else 0.0
+        self.init_score = init if abs(init) > K_EPSILON else 0.0
+        self.finished = False          # TrainOneIter returned true: no tree could split (gbdt.cpp:448-456)
         score0 = np.full(self.n, self.init_score, dtype=np.float64)
         if device_resident:
             self.d_label = DeviceArray(self.n * 4).upload(self.label)
@@ -124,21 +123,50 @@ class B200Booster:
             t2 = time.perf_counter()
             self.host_ms["gradients"] += (t1 - t0) * 1e3
             self.host_ms["train"] += (t2 - t1) * 1e3
+        if tree.num_leaves <= 1:
+            return self._no_split(tree)
         tree.shrinkage(self.lr)
-        if tree.num_leaves > 1:
-            if self.device_resident:
-                if self.goss and len(self.trees) >= int(1.0 / self.lr):
-                    self.learner.add_prediction_all_rows(tree, self.d_score)      # out-of-bag rows are scored too (gbdt.cpp:505-530)
-                else:
-                    self.learner.add_prediction_to_score(tree, self.d_score)
+        if self.device_resident:
+            if self.goss and len(self.trees) >= int(1.0 / self.lr):
+                self.learner.add_prediction_all_rows(tree, self.d_score)      # out-of-bag rows are scored too (gbdt.cpp:505-530)
             else:
-                t3 = time.perf_counter()
-                self.learner.add_prediction_to_score(tree, self.score)
-                self.host_ms["score"] += (time.perf_counter() - t3) * 1e3
+                self.learner.add_prediction_to_score(tree, self.d_score)
+        else:
+            t3 = time.perf_counter()
+            self.learner.add_prediction_to_score(tree, self.score)
+            self.host_ms["score"] += (time.perf_counter() - t3) * 1e3
         if not self.trees and self.init_score != 0.0:
             tree.add_bias(self.init_score)     # gbdt.cpp:424-427 (first tree carries the average)
         self.trees.append(tree)
         return tree
+
+    def _no_split(self, tree: Tree) -> Tree:
+        """TrainOneIter when the tree cannot split (gbdt.cpp:427-456): the first tree becomes the constant init score, a
+        later one is the constant 0 and is dropped; either way training has finished."""
+        if self.trees:
+            tree.as_constant(0.0, self.n)
+        else:
+            init = self.init_score
+            if not self.boost_from_average:
+                # the init score the scores never started from is added now, whatever its size
+                init = self._automatic_init_score()
+                if self.device_resident:
+                    self.d_score.upload(self.scores() + init)
+                else:
+                    self.score += init
+            tree.as_constant(init, self.n)
+            self.trees.append(tree)
+        self.finished = True
+        return tree
+
+    def _automatic_init_score(self) -> float:
+        """ObjectiveFunction::BoostFromScore: RegressionL2loss the mean label; BinaryLogloss log(p / (1 - p)) / sigmoid
+        with p clamped to [kEpsilon, 1 - kEpsilon] (binary_objective.hpp:139-165)."""
+        if self.objective == "regression":
+            return float(np.mean(self.label, dtype=np.float64))
+        pavg = float(np.count_nonzero(self.label > 0)) / self.n
+        pavg = max(min(pavg, 1.0 - K_EPSILON), K_EPSILON)
+        return math.log(pavg / (1.0 - pavg)) / self.sigmoid
 
     def update_custom(self, grad, hess) -> Tree:
         """LGBM_BoosterUpdateOneIterCustom (c_api.h:801): caller-provided gradients."""
@@ -246,4 +274,6 @@ def train(params: dict, train_set, num_boost_round: int = 100) -> B200Booster:
                     other_rate=float(p.get("other_rate", 0.1)), bagging_seed=int(p.get("bagging_seed", 3)))
     for _ in range(num_boost_round):
         b.update()
+        if b.finished:
+            break
     return b

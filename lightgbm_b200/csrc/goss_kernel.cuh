@@ -103,7 +103,7 @@ __global__ void __launch_bounds__(kGossThreads) k_goss_mark(const GossArgs a) {
     if (i < hi) {
       const float g = a.grad[i], h = a.hess[i];
       if (goss_key(g, h) >= s.threshold_key) keep = true;
-      else if (quant_uniform(a.seed, a.iter, static_cast<unsigned>(i), 2u) < static_cast<double>(s.prob)) {
+      else if (quant_uniform(a.seed, a.iter, static_cast<unsigned>(i), kGossStream) < static_cast<double>(s.prob)) {
         keep = true;
         a.grad[i] = g * s.multiply; a.hess[i] = h * s.multiply;          // goss.hpp:157-158
       }

@@ -192,6 +192,9 @@ class Learner {
     CUDA_CHECK(cudaFuncSetAttribute(k_hist_a<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, AShape<false>::kSmem));
     CUDA_CHECK(cudaFuncSetAttribute(k_hist_q, cudaFuncAttributeMaxDynamicSharedMemorySize, kQSmemBytes));
     CUDA_CHECK(cudaFuncSetAttribute(k_hist_q, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+    // RouteAllRows stages up to kRouteMaxSplits records (53 248 B), past the 48 KB a launch gets without opting in
+    CUDA_CHECK(cudaFuncSetAttribute(k_route_rows, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    static_cast<int>(sizeof(RouteSplit) * kRouteMaxSplits)));
     BuildTensorMap();
     inited_ = true;
     AllocTreeState();

@@ -495,8 +495,11 @@ __global__ void __launch_bounds__(32) k_quant_scales(const PrepArgs a) {
   c->quant_iter += 1;
 }
 
-// counter-based uniform in [0,1) for stochastic rounding (splitmix64 finaliser over (seed, tree, row, stream))
-__device__ __forceinline__ double quant_uniform(unsigned long long seed, unsigned long long iter, unsigned row, unsigned stream) {
+// counter-based uniform in [0,1) (splitmix64 finaliser over (seed, tree, row, stream)).  The counter is
+// row << 1 | stream: stochastic rounding draws on streams 0 and 1, which fill bit 0.  Rows are below 2^31, so those
+// counters stay below 2^32, and GOSS draws on kGossStream, the bit above them: every (row, stream) has its own counter.
+constexpr unsigned long long kGossStream = 1ull << 32;
+__device__ __forceinline__ double quant_uniform(unsigned long long seed, unsigned long long iter, unsigned row, unsigned long long stream) {
   unsigned long long z = seed * 0x9E3779B97F4A7C15ull + iter * 0xBF58476D1CE4E5B9ull + (static_cast<unsigned long long>(row) << 1 | stream);
   z += 0x9E3779B97F4A7C15ull;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;

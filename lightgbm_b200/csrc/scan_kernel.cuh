@@ -16,7 +16,8 @@
 // Tie consistency: in the reference two thresholds separated by an EMPTY bin give bit-identical sums
 // and the first in scan order wins.  A parallel prefix is not bit-consistent across lanes, so the
 // rule is applied explicitly: a candidate whose just-accumulated bin is empty is a duplicate of the
-// previous candidate and is skipped.  With the int64 pool an empty bin is exactly (0,0).
+// previous candidate and is skipped.  With the int64 pool an empty bin is exactly (0,0).  A bin whose rows all have
+// hessian 0 (a saturated logistic) is (g, 0) with g != 0: it is not empty, and its gradient counts like any other.
 #pragma once
 #include "comm.cuh"
 #include "types.cuh"
@@ -586,7 +587,7 @@ __global__ void __launch_bounds__(kScanWarps * 32, ROWS ? 1 : 2) k_scan(const __
       if (which == 0) {
         const Leaf& LS = a.leaves[smaller];
 #pragma unroll
-        for (int k = 0; k < 8; ++k) { h[k] = static_cast<double>(ih[k]) * h_inv; g[k] = (ih[k] == 0) ? 0.0 : static_cast<double>(ig[k]) * g_inv; }
+        for (int k = 0; k < 8; ++k) { h[k] = static_cast<double>(ih[k]) * h_inv; g[k] = static_cast<double>(ig[k]) * g_inv; }
         sum_g = LS.sum_g; sum_h = LS.sum_h; cnt = LS.count;
         po = (c->num_leaves == 1)
             ? leaf_output(GainCfg{1, 1, 0, a.params.l1, a.params.l2, a.params.max_delta_step, a.params.path_smooth}, LS.sum_g, LS.sum_h, LS.count, 0.0)
@@ -603,7 +604,7 @@ __global__ void __launch_bounds__(kScanWarps * 32, ROWS ? 1 : 2) k_scan(const __
             v.x -= ig[k]; v.y -= ih[k];
             *reinterpret_cast<longlong2*>(hl + 2 * e) = v;
             h[k] = static_cast<double>(v.y) * h_inv;
-            g[k] = (v.y == 0) ? 0.0 : static_cast<double>(v.x) * g_inv;
+            g[k] = static_cast<double>(v.x) * g_inv;
           } else { g[k] = 0.0; h[k] = 0.0; }
         }
         sum_g = LL.sum_g; sum_h = LL.sum_h; cnt = LL.count; po = LL.output;

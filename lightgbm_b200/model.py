@@ -17,16 +17,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from ._lib import check, lib
-from .tree_learner import Layout, Tree, _p
-
-K_ZERO = float(np.float32(1e-35))            # kZeroThreshold (meta.h:56)
-
-
-def _round_to_zero(a: np.ndarray) -> np.ndarray:
-    """Tree::MaybeRoundToZero (tree.h:318-320)."""
-    a = np.asarray(a, np.float64).copy()
-    a[np.abs(a) <= K_ZERO] = 0.0
-    return a
+from .tree_learner import Layout, Tree, _p, round_to_zero
 
 
 def _g(x) -> str:
@@ -70,7 +61,7 @@ class ModelTree:
         sf = np.zeros(n, np.int32); sg = np.zeros(n, np.float32); th = np.zeros(n, np.float64); dt = np.zeros(n, np.int8)
         lc = np.zeros(n, np.int32); rc = np.zeros(n, np.int32)
         iv = np.zeros(n, np.float64); iw = np.zeros(n, np.float64); ic = np.zeros(n, np.int32)
-        value = np.zeros(L, np.float64); weight = np.zeros(L, np.float64); count = np.zeros(L, np.int32)
+        value = np.zeros(L, np.float64)
         parent = np.full(L, -1, np.int64)
         for node in range(n):
             s = t.splits[node]
@@ -94,13 +85,11 @@ class ModelTree:
             lo, ro = float(s["left_output"]), float(s["right_output"])
             value[leaf] = 0.0 if np.isnan(lo) else lo
             value[new_leaf] = 0.0 if np.isnan(ro) else ro
-            weight[leaf], weight[new_leaf] = s["left_sum_hessian"], s["right_sum_hessian"]
-            count[leaf], count[new_leaf] = s["left_count"], s["right_count"]
-        iv = _round_to_zero(iv * shrinkage)
+        iv = round_to_zero(iv * shrinkage)
         if bias != 0.0:
-            iv = _round_to_zero(iv + bias)
-        return ModelTree(L, sf, sg, th, dt, lc, rc, _round_to_zero(t.leaf_value), np.asarray(t.leaf_weight, np.float64).copy() if n else weight,
-                         np.asarray(t.leaf_count, np.int32).copy() if n else count, iv, iw, ic,
+            iv = round_to_zero(iv + bias)
+        return ModelTree(L, sf, sg, th, dt, lc, rc, round_to_zero(t.leaf_value), np.asarray(t.leaf_weight, np.float64).copy(),
+                         np.asarray(t.leaf_count, np.int32).copy(), iv, iw, ic,
                          shrinkage=1.0 if bias != 0.0 else float(shrinkage))
 
     # Tree::ToString

@@ -152,14 +152,33 @@ class Tree:
     bias: float = 0.0                # the internal node values (lightgbm_b200/model.py)
 
     def shrinkage(self, rate: float) -> None:
-        """Tree::Shrinkage (reference include/LightGBM/tree.h:187-200)."""
-        self.leaf_value = self.leaf_value * rate
+        """Tree::Shrinkage (reference include/LightGBM/tree.h:187-200): leaf values in the zero band become 0, so the
+        score update adds what the model text holds."""
+        self.leaf_value = round_to_zero(self.leaf_value * rate)
         self.shrink *= rate
 
     def add_bias(self, val: float) -> None:
         """Tree::AddBias (reference tree.h:211-230)."""
-        self.leaf_value = self.leaf_value + val
+        self.leaf_value = round_to_zero(self.leaf_value + val)
         self.bias += val
+
+    def as_constant(self, val: float, count: int) -> None:
+        """Tree::AsConstantTree (tree.h:232-240): one leaf holding `val`, weight 0, `count` rows, shrinkage 1."""
+        self.num_leaves = 1
+        self.splits = self.splits[:0]
+        self.leaf_value, self.leaf_weight = np.array([float(val)]), np.zeros(1)
+        self.leaf_count, self.leaf_depth = np.array([count], np.int32), np.zeros(1, np.int32)
+        self.shrink, self.bias = 1.0, 0.0
+
+
+K_ZERO = float(np.float32(1e-35))            # kZeroThreshold (meta.h:56): the float literal, widened
+
+
+def round_to_zero(a) -> np.ndarray:
+    """Tree::MaybeRoundToZero (tree.h:258-260) on every element: |v| <= kZeroThreshold becomes 0."""
+    a = np.array(a, np.float64)
+    a[np.abs(a) <= K_ZERO] = 0.0
+    return a
 
 
 def _p(a):

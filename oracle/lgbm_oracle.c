@@ -645,11 +645,11 @@ int orc_train_tree(const OrcLayout* L, const uint8_t* bins, const float* grad, c
 
 int orc_train_tree_quant(const OrcLayout* L, const uint8_t* bins, const float* grad, const float* hess,
                          const int32_t* bag_indices, int32_t bag_count, const uint8_t* feature_used,
-                         const OrcParams* P, OrcQuant* Q, OrcTree* T) {
+                         const OrcParams* P, OrcQuant* Q, const double* random_g, const double* random_h, OrcTree* T) {
   float* qg = (float*)malloc(sizeof(float) * (size_t)L->num_data);
   float* qh = (float*)malloc(sizeof(float) * (size_t)L->num_data);
   if (!qg || !qh) return -1;
-  orc_discretize(grad, hess, L->num_data, Q, NULL, NULL, qg, qh);
+  orc_discretize(grad, hess, L->num_data, Q, random_g, random_h, qg, qh);
   const int rc = train_impl(L, bins, qg, qh, bag_indices, bag_count, feature_used, P, T, Q, grad, hess);
   free(qg); free(qh);
   return rc;

@@ -138,7 +138,7 @@ int orc_find_best_threshold_int(const OrcLayout* L, const OrcParams* P, int feat
  * hess_scale are filled in. */
 int orc_train_tree_quant(const OrcLayout* L, const uint8_t* bins, const float* grad, const float* hess,
                          const int32_t* bag_indices, int32_t bag_count, const uint8_t* feature_used,
-                         const OrcParams* P, OrcQuant* Q, OrcTree* out);
+                         const OrcParams* P, OrcQuant* Q, const double* random_g, const double* random_h, OrcTree* out);
 
 #ifdef __cplusplus
 }

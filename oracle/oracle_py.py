@@ -152,8 +152,9 @@ def discretize(grad, hess, num_grad_quant_bins=4, is_constant_hessian=False, ran
 
 
 def train_tree_quant(lay, grad, hess, num_grad_quant_bins=4, is_constant_hessian=False, renew_leaf=False,
-                     bag_indices=None, feature_used=None, **params) -> OracleTree:
-    """SerialTreeLearner::Train with use_quantized_grad=true, stochastic_rounding=false."""
+                     bag_indices=None, feature_used=None, random_g=None, random_h=None, **params) -> OracleTree:
+    """SerialTreeLearner::Train with use_quantized_grad=true: stochastic_rounding=false, or the per-row uniforms of
+    stochastic rounding in random_g / random_h (as discretize() takes them)."""
     L, keep = make_layout(lay)
     P = make_params(**params)
     NL = P.num_leaves
@@ -168,9 +169,12 @@ def train_tree_quant(lay, grad, hess, num_grad_quant_bins=4, is_constant_hessian
     Q = _OrcQuant(num_grad_quant_bins, 1 if is_constant_hessian else 0, 1 if renew_leaf else 0, 0.0, 0.0)
     bag = None if bag_indices is None else np.ascontiguousarray(bag_indices, dtype=np.int32)
     fu = None if feature_used is None else np.ascontiguousarray(feature_used, dtype=np.uint8)
+    rg = None if random_g is None else np.ascontiguousarray(random_g, dtype=np.float64)
+    rh = None if random_h is None else np.ascontiguousarray(random_h, dtype=np.float64)
     r = lib().orc_train_tree_quant(C.byref(L), _p(bins), _p(g), _p(h), None if bag is None else _p(bag),
                                    C.c_int32(0 if bag is None else len(bag)), None if fu is None else _p(fu),
-                                   C.byref(P), C.byref(Q), C.byref(T))
+                                   C.byref(P), C.byref(Q), None if rg is None else _p(rg), None if rh is None else _p(rh),
+                                   C.byref(T))
     if r != 0:
         raise RuntimeError("orc_train_tree_quant failed")
     n = T.num_leaves

@@ -465,3 +465,102 @@ def binner_columns(meta, ub, ncol, float64):
         nb, mt = int(meta["feat_num_bin"][f]), int(meta["feat_missing_type"][f])
         cols[int(meta["feat_real_index"][f])] = boundary_values(ub[f][:nb - 1 - (1 if mt == MISSING_NAN else 0)], float64)
     return cols
+
+
+# ---- plain restatements of one boosting iteration (DESIGN.md §2, §4.7) ----------------------------------------------
+# Everything between one tree and the next is deterministic: the objective's gradients, GOSS (its draws come from a
+# counter, not a sequential generator), the stochastic rounding uniforms and the score update.  These restate each of
+# them in float64 / uint64 numpy; transcendental functions go through Python's math (libm), since numpy may evaluate
+# exp / log with SIMD code that rounds differently.
+
+QUANT_G_STREAM, QUANT_H_STREAM = 0, 1      # stochastic rounding of gradients / hessians (partition_kernel.cuh quantize_row)
+GOSS_STREAM = 1 << 32                      # GOSS draws (goss_kernel.cuh k_goss_mark): above every row << 1 | 1
+_M64 = (1 << 64) - 1
+
+
+def counter_uniform(seed, iteration, rows, stream) -> np.ndarray:
+    """quant_uniform (partition_kernel.cuh): the splitmix64 finaliser over the counter seed * phi + iteration * c1 +
+    (row << 1 | stream), with wrapping uint64 arithmetic, as a double in [0, 1) from the top 53 bits.  One independent
+    value per (seed, iteration, row, stream) for stream in {QUANT_G_STREAM, QUANT_H_STREAM, GOSS_STREAM}.  The device
+    takes seed and iteration as 32-bit unsigned values."""
+    rows = np.asarray(rows, np.int64).astype(np.uint64)
+    base = ((int(seed) & 0xFFFFFFFF) * 0x9E3779B97F4A7C15 + (int(iteration) & 0xFFFFFFFF) * 0xBF58476D1CE4E5B9) & _M64
+    z = np.uint64(base) + ((rows << np.uint64(1)) | np.uint64(stream))
+    z = z + np.uint64(0x9E3779B97F4A7C15)
+    z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+    z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    z = z ^ (z >> np.uint64(31))
+    return (z >> np.uint64(11)).astype(np.float64) * (1.0 / 9007199254740992.0)
+
+
+def goss_reference(g, h, top_rate, other_rate, seed, iteration):
+    """GOSS as k_goss_begin / pick / mark / scatter compute it.  top_k = max(1, int(n * top_rate)) and
+    other_k = int(n * other_rate); the threshold is the top_k-th largest float |g * h|; a row at or above it is kept
+    as is; any other row is kept when its GOSS_STREAM uniform is below prob = float(other_k / (n - top_k)), compared as a
+    double, and then its g and h are multiplied by the float (n - top_k) / other_k.  Returns (ascending bag, g', h')."""
+    g = np.asarray(g, np.float32)
+    h = np.asarray(h, np.float32)
+    n = len(g)
+    top_k = max(1, int(n * float(top_rate)))
+    other_k = int(n * float(other_rate))
+    multiply = np.float32(n - top_k) / np.float32(other_k) if other_k > 0 else np.float32(0.0)
+    prob = float(np.float32(other_k / (n - top_k))) if n - top_k > 0 else 0.0
+    key = np.abs(g * h).view(np.uint32)
+    thr = np.sort(key)[n - top_k]                       # the top_k-th largest bit pattern (uint order == float order)
+    top = key >= thr
+    drawn = ~top & (counter_uniform(seed, iteration, np.arange(n), GOSS_STREAM) < prob)
+    g2, h2 = g.copy(), h.copy()
+    g2[drawn] = g[drawn] * multiply
+    h2[drawn] = h[drawn] * multiply
+    return np.nonzero(top | drawn)[0].astype(np.int32), g2, h2
+
+
+def l2_gradients_reference(score, label):
+    """k_l2_gradients (regression_objective.hpp:127-142, unweighted): g = float(score - label) in double, h = 1."""
+    g = (np.asarray(score, np.float64) - np.asarray(label, np.float32).astype(np.float64)).astype(np.float32)
+    return g, np.ones(len(g), np.float32)
+
+
+def binary_gradients_reference(score, label, sigmoid):
+    """k_binary_gradients (binary_objective.hpp:105-121, unweighted): with lab = +-1,
+    response = -lab * sigmoid / (1 + exp(lab * sigmoid * score)), g = float(response),
+    h = float(|response| * (sigmoid - |response|)); exp through libm, inf where it overflows."""
+    score = np.asarray(score, np.float64)
+    label = np.asarray(label, np.float32)
+    g, h = np.empty(len(score), np.float32), np.empty(len(score), np.float32)
+    for i, (s, y) in enumerate(zip(score.tolist(), label.tolist())):
+        lab = 1 if y > 0.0 else -1
+        try:
+            e = math.exp(lab * sigmoid * s)
+        except OverflowError:
+            e = math.inf
+        response = -lab * sigmoid / (1.0 + e)
+        ar = abs(response)
+        g[i], h[i] = response, ar * (sigmoid - ar)
+    return g, h
+
+
+def route_rows_reference(layout, splits, rows=None) -> np.ndarray:
+    """int32 leaf of every row in `rows` (default all) of `layout` after the split records `splits`, applied in order
+    (Tree::Split, tree.h:543-585): a row in leaf s.leaf when split i is applied moves to leaf i + 1 unless the oracle's
+    partition rule (DataPartition::Split) sends it left."""
+    from oracle import oracle_py
+    rows = np.arange(layout.num_data, dtype=np.int32) if rows is None else np.asarray(rows, np.int32)
+    leaf = np.zeros(layout.num_data, np.int32)
+    for i, s in enumerate(splits):
+        here = rows[leaf[rows] == int(s["leaf"])]
+        if len(here) == 0:
+            continue
+        idx, nl = oracle_py.partition(layout, int(s["feature"]), int(s["threshold"]), int(s["default_left"]), here)
+        leaf[idx[nl:]] = i + 1
+    out = np.full(layout.num_data, -1, np.int32)
+    out[rows] = leaf[rows]
+    return out
+
+
+def boost_step_reference(score, leaf_value, row_leaf) -> np.ndarray:
+    """score + leaf_value[leaf of the row] in float64, for every row with a leaf (row_leaf >= 0); others untouched."""
+    out = np.array(score, np.float64)
+    m = np.asarray(row_leaf) >= 0
+    out[m] += np.asarray(leaf_value, np.float64)[np.asarray(row_leaf)[m]]
+    return out

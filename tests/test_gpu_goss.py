@@ -1,17 +1,19 @@
 """GPU: GOSS on the device (lightgbm_b200/csrc/goss_kernel.cuh) against the definition of GOSSStrategy::Helper
-(reference src/boosting/goss.hpp:118-167): exact where the reference is deterministic (threshold, scaling, ordering),
-statistical where it draws random numbers; and the tree grown on the sampled set equals the oracle's tree on the same
-set and the same rescaled gradients."""
+(reference src/boosting/goss.hpp:118-167), byte for byte against tests/helpers.py goss_reference, whose draws are the
+device's counter-based uniforms (tests/test_gpu_boosting_exact.py covers the edge sizes, keys and rates); and the tree
+grown on the sampled set equals the oracle's tree on the same set and the same rescaled gradients."""
 import numpy as np
 import pytest
 
-from helpers import compare_trees, synth_identity
+from helpers import compare_trees, goss_reference, synth_identity
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("n,top,other", [(200_000, 0.2, 0.1), (50_001, 0.05, 0.3), (1000, 0.5, 0.5)])
 def test_goss_sample_definition(built_lib, n, top, other):
+    """The bag and the rescaled arrays equal the restatement byte for byte (tests/helpers.py goss_reference); the same
+    iteration draws the same bag, another iteration another."""
     import lightgbm_b200 as lgb
     from lightgbm_b200.tree_learner import DeviceArray
     bins, y, g, h = synth_identity(n, 8, seed=n)
@@ -22,30 +24,16 @@ def test_goss_sample_definition(built_lib, n, top, other):
     dg, dh = DeviceArray(n * 4).upload(g), DeviceArray(n * 4).upload(h)
     cnt = L.goss_sample(dg, dh, top, other, seed=7, iteration=11)
     bag = L.get_bagging_data(cnt)
-    g2, h2 = dg.download(np.float32, n), dh.download(np.float32, n)
-    assert np.all(np.diff(bag) > 0)                                   # ascending, no duplicates
-    key = np.abs(g * h)
-    top_k, other_k = max(1, int(n * top)), int(n * other)
-    thr = np.partition(key, n - top_k)[n - top_k]                     # ArgMaxAtK(top_k - 1): the k-th largest
-    is_top = key >= thr
-    in_bag = np.zeros(n, bool); in_bag[bag] = True
-    assert np.all(in_bag[is_top])                                     # every row at or above the threshold is kept (goss.hpp:147)
-    drawn = in_bag & ~is_top
-    mult = np.float32((n - top_k) / other_k)
-    np.testing.assert_array_equal(g2[drawn], g[drawn] * mult)         # goss.hpp:157-158
-    np.testing.assert_array_equal(h2[drawn], h[drawn] * mult)
-    np.testing.assert_array_equal(g2[~drawn], g[~drawn])              # top rows and dropped rows are untouched
-    np.testing.assert_array_equal(h2[~drawn], h[~drawn])
-    # number drawn ~ Binomial(n - #top, other_k / (n - top_k))
-    m, p = int((~is_top).sum()), other_k / (n - top_k)
-    assert abs(int(drawn.sum()) - m * p) <= 6 * np.sqrt(m * p * (1 - p)) + 2
-    # a different iteration draws a different subset, the same iteration the same one
+    want_bag, want_g, want_h = goss_reference(g, h, top, other, 7, 11)
+    assert bag.tobytes() == want_bag.tobytes()
+    assert dg.download(np.float32, n).tobytes() == want_g.tobytes()
+    assert dh.download(np.float32, n).tobytes() == want_h.tobytes()
     dg.upload(g); dh.upload(h)
     cnt2 = L.goss_sample(dg, dh, top, other, seed=7, iteration=11)
     assert cnt2 == cnt and np.array_equal(L.get_bagging_data(cnt2), bag)
     dg.upload(g); dh.upload(h)
     cnt3 = L.goss_sample(dg, dh, top, other, seed=7, iteration=12)
-    assert not np.array_equal(L.get_bagging_data(cnt3), bag) or cnt3 == n
+    assert L.get_bagging_data(cnt3).tobytes() == goss_reference(g, h, top, other, 7, 12)[0].tobytes()
 
 
 def test_tree_on_goss_sample_matches_oracle(built_lib):

@@ -116,7 +116,7 @@ def test_raw_floats_to_model_text_to_reference_predict(built_lib, objective):
     Xt = r.normal(size=(5000, f)).astype(np.float32); Xt[r.random((5000, f)) < 0.05] = np.nan
     mine = m.predict_raw(Xt)
     # the training scores the booster kept on the device are the model's predictions on the training matrix
-    np.testing.assert_allclose(m.predict_raw(X), bst.scores(), rtol=1e-12, atol=1e-12)
+    assert m.predict_raw(X).tobytes() == bst.scores().tobytes()
     assert lgb.Model.from_string(text).predict_raw(Xt).tobytes() == mine.tobytes()
     if refapi.available():
         loaded = refapi.RefLoadedBooster(text)
